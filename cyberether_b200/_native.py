@@ -89,6 +89,9 @@ SIGNATURES = {
     "b200_fir_reset": (c_int, [c_vp, c_vp]),
     "b200_fir_set_history": (c_int, [c_vp, c_vp, c_u64, c_u64, c_vp]),
     "b200_fir_plan_destroy": (c_int, [c_vp]),
+    "b200_fold": (c_int, [c_vp, c_vp, c_vp, c_int, c_u64, c_u64, c_u64, c_u64, c_u64, c_vp, c_u64, c_u64, c_vp]),
+    "b200_overlap_add": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_u64, c_u64, c_u64, c_u64, c_u64, c_u64, c_vp]),
+    "b200_phase_correction": (c_int, [c_vp, c_vp, c_vp, c_u64, c_u64, c_u64, c_u64, c_u64, P(c_f64), P(c_f64), c_vp]),
     "b200_fm_plan_create": (c_int, [c_vp, c_u64, c_f32, c_int, c_int, P(c_vp)]),
     "b200_fm_exec": (c_int, [c_vp, c_vp, c_vp, c_u64, c_u64, c_vp]),
     "b200_fm_reset": (c_int, [c_vp, c_vp]),

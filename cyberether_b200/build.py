@@ -10,7 +10,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(CSRC, "_obj")
-SOURCES = ["context.cu", "elementwise.cu", "fft.cu", "fir.cu", "fm.cu", "agc.cu", "viz.cu"]
+SOURCES = ["context.cu", "elementwise.cu", "fft.cu", "fir.cu", "fm.cu", "agc.cu", "viz.cu", "filter_stages.cu"]
 OUT = os.path.join(HERE, "libb200dsp.so")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC"]

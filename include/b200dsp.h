@@ -339,6 +339,47 @@ int b200_fir_set_history(b200_fir_plan* plan, const b200_cf32* tail_dev, uint64_
                          b200_stream stream);
 int b200_fir_plan_destroy(b200_fir_plan* plan);
 
+/* The separate stages of the filter / filter_engine wiring (src/domains/dsp/filter/block_impl.cc:350-582), for the
+ * layouts the fused FIR does not take and for flowgraphs wired by hand. pad and unpad are b200_copy_strided calls. */
+
+/* fold — FoldImplNativeCpu::foldKernel, src/domains/dsp/fold/module_impl_native_cpu.cc:102-172 (validation and offsets:
+ * src/domains/dsp/fold/module_impl.cc:8-113). in: contiguous [outer, axis, inner], out: contiguous [outer, size, inner],
+ * F32 (is_complex = 0) or CF32; `size` divides `axis`, R = axis / size:
+ *   out[r, o, i] = (1/R) sum_{g < R} in[r, (o + g size - offset) mod axis, i]
+ * summed in F64 in ascending g, divided by R in F64 and rounded once: bit-identical to the reference. `offset` is the
+ * module's scalar offset; with `channel_offsets` (device pointer, `channels` U64 values, the input's "channelOffsets"
+ * attribute) output element k uses channel_offsets[(k / channel_inner) % channels] instead. Offsets are taken mod axis.
+ * Stateless. */
+int b200_fold(b200_ctx* ctx, const void* in, void* out, int is_complex, uint64_t outer, uint64_t axis, uint64_t inner,
+              uint64_t size, uint64_t offset, const uint64_t* channel_offsets, uint64_t channels,
+              uint64_t channel_inner, b200_stream stream);
+
+/* overlap_add — OverlapAddImplNativeCpu, src/domains/dsp/overlap_add/module_impl_native_cpu.cc:120-202. buffer / out:
+ * contiguous [outer, buffer_len, inner]; overlap: contiguous [outer, overlap_len, inner], overlap_len <= buffer_len;
+ * F32 (is_complex = 0) or CF32. The batch coordinate of overlap element k is (k / batch_stride) % batches (batches = 1
+ * without a batch axis). out = buffer, and over the first overlap_len samples of every row out += the previous batch's
+ * overlap, or for batch 0 the carried `previous` tail ([overlap with the batch extent reduced to 1], device memory
+ * owned by the caller, zero before the first call). Then `previous` = the last batch of overlap. One F32 add per
+ * element: bit-identical to the reference. Two launches on `stream`, so the read of the old tail is ordered before its
+ * overwrite; `previous` must not alias the other tensors. */
+int b200_overlap_add(b200_ctx* ctx, const void* buffer, const void* overlap, void* out, void* previous, int is_complex,
+                     uint64_t outer, uint64_t buffer_len, uint64_t overlap_len, uint64_t inner, uint64_t batches,
+                     uint64_t batch_stride, b200_stream stream);
+
+/* phase_correction — PhaseCorrectionImplNativeCpu::computeSubmit, src/domains/dsp/phase_correction/
+ * module_impl_native_cpu.cc:81-115. in / out: contiguous CF32, `count` elements; element k belongs to batch
+ * (k / batch_inner) % batches and channel (k / channel_inner) % channels (batches = 1 / channels = 1 without the axis)
+ * and is multiplied, with std::complex<float>'s operation order, by (cos phi, sin phi) rounded to F32 from
+ *   phi = phases[channel] + wrapped_increments[channel] * batch      (F64, no FMA)
+ * `phases` and `wrapped_increments` are HOST arrays of `channels` values, passed to the kernel by value: the caller
+ * keeps the per-channel phase on the host and advances it after each call as the reference does
+ * (phases[c] = remainder(phases[c] + wrapped[c] * batches, 2 pi)). Differs from the reference only where CUDA's F64
+ * cos / sin and glibc's round to different F32 values. At most B200_PHASE_CORRECTION_MAX_CHANNELS channels. */
+#define B200_PHASE_CORRECTION_MAX_CHANNELS 128
+int b200_phase_correction(b200_ctx* ctx, const b200_cf32* in, b200_cf32* out, uint64_t count, uint64_t batches,
+                          uint64_t batch_inner, uint64_t channels, uint64_t channel_inner, const double* phases,
+                          const double* wrapped_increments, b200_stream stream);
+
 /* ---- fm ---------------------------------------------------------------------------------------- */
 
 /* fm — FmImplNativeCpu::computeSubmit, src/domains/dsp/fm/module_impl_native_cpu.cc:43-175, coefficients of

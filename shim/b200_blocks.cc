@@ -24,6 +24,19 @@
 #include "domains/dsp/filter/block_impl.cc"            // NOLINT(bugprone-suspicious-include)
 #pragma pop_macro("JST_REGISTER_BLOCK")
 
+// Blocks this provider runs with the reference's own wiring and registration, unchanged: the filter_engine channeliser
+// and the single-module blocks of a hand-wired overlap-add flowgraph (examples/flowgraphs/overlap-add-fold.yml). Their
+// modules are the reference's CPU modules and the b200 modules of shim/b200_modules.cc.
+#include "domains/dsp/filter_engine/block_impl.cc"     // NOLINT(bugprone-suspicious-include)
+#include "domains/dsp/filter_taps/block_impl.cc"       // NOLINT(bugprone-suspicious-include)
+#include "domains/dsp/fold/block_impl.cc"              // NOLINT(bugprone-suspicious-include)
+#include "domains/dsp/overlap_add/block_impl.cc"       // NOLINT(bugprone-suspicious-include)
+#include "domains/dsp/phase_correction/block_impl.cc"  // NOLINT(bugprone-suspicious-include)
+#include "domains/core/pad/block_impl.cc"              // NOLINT(bugprone-suspicious-include)
+#include "domains/core/unpad/block_impl.cc"            // NOLINT(bugprone-suspicious-include)
+#include "domains/core/multiply/block_impl.cc"         // NOLINT(bugprone-suspicious-include)
+#include "domains/core/expand_dims/block_impl.cc"      // NOLINT(bugprone-suspicious-include)
+
 namespace Jetstream::Blocks {
 
 namespace {

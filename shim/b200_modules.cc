@@ -29,14 +29,19 @@
 #include "domains/core/expand_dims/module_impl.hh"
 #include "domains/core/multiply/module_impl.hh"
 #include "domains/core/multiply_constant/module_impl.hh"
+#include "domains/core/pad/module_impl.hh"
 #include "domains/core/range/module_impl.hh"
 #include "domains/core/reshape/module_impl.hh"
+#include "domains/core/unpad/module_impl.hh"
 #include "domains/dsp/agc/module_impl.hh"
 #include "domains/dsp/amplitude/module_impl.hh"
 #include "domains/dsp/fft/module_impl.hh"
 #include "domains/dsp/filter_taps/module_impl.hh"
 #include "domains/dsp/fm/module_impl.hh"
+#include "domains/dsp/fold/module_impl.hh"
 #include "domains/dsp/invert/module_impl.hh"
+#include "domains/dsp/overlap_add/module_impl.hh"
+#include "domains/dsp/phase_correction/module_impl.hh"
 #include "domains/dsp/window/module_impl.hh"
 #include "domains/visualization/lineplot/module_impl.hh"
 #include "domains/visualization/waterfall/module_impl.hh"
@@ -140,22 +145,53 @@ JST_REGISTER_MODULE(MultiplyImplB200, DeviceType::CUDA, RuntimeType::NATIVE, "b2
 // CF32 -> CF32 (either direction) through b200_fft_exec; F32 input, forward (pocketfft::r2c with `complexOutput`, else
 // r2r_fftpack: src/domains/dsp/fft/module_impl_native_cpu.cc:142-167) through b200_fft_exec_real — one complex transform of
 // half the length on the real row itself plus the unpack kernel.
+// A CF32 transform along another axis, or over a strided view (the module is DISCONTIGUOUS), gathers the rows into a
+// contiguous [rows, n] scratch with b200_copy_strided, transforms it in place and scatters it into the output — what the
+// reference's CUDA module does with its fft_layout kernel (module_impl_native_cuda.cc:31-141).
 struct FftImplB200 : public FftImpl, public NativeCudaRuntimeContext, public Scheduler::Context {
     Result create() final {
         JST_CHECK(FftImpl::create());
-        if (!input.contiguous() || resolvedAxis + 1 != input.rank()) {
-            JST_ERROR("[MODULE_FFT_B200] This provider implements contiguous transforms along the innermost axis.");
-            return Result::ERROR;
-        }
         const U64 n = input.shape(resolvedAxis);
         realInput = input.dtype() == DataType::F32;
         if (input.dtype() != DataType::CF32 && !realInput) {
             JST_ERROR("[MODULE_FFT_B200] Unsupported input data type.");
             return Result::ERROR;
         }
+        const bool innermost = input.contiguous() && resolvedAxis + 1 == input.rank();
+        if (realInput && !innermost) {
+            JST_ERROR("[MODULE_FFT_B200] Real input: this provider implements contiguous transforms along the innermost axis.");
+            return Result::ERROR;
+        }
         if (realInput && (!forward || n < 4 || n % 2 != 0)) {
             JST_ERROR("[MODULE_FFT_B200] Real input: this provider implements the forward transform of even lengths >= 4.");
             return Result::ERROR;
+        }
+        gatherShape.clear();
+        inputStride.clear();
+        outputStride.clear();
+        rows = Tensor();
+        if (!innermost) {
+            if (input.rank() > 8) {
+                JST_ERROR("[MODULE_FFT_B200] Rank {} exceeds the supported 8.", input.rank());
+                return Result::ERROR;
+            }
+            // input / output dimensions in the order (every other axis, transform axis); scratch strides row-major
+            const auto& inStride = input.stride();
+            const auto& outStride = output.stride();
+            for (Index d = 0; d <= input.rank(); ++d) {
+                const Index dim = d == input.rank() ? resolvedAxis : d;
+                if (d == resolvedAxis) {
+                    continue;
+                }
+                gatherShape.push_back(input.shape(dim));
+                inputStride.push_back(inStride[dim]);
+                outputStride.push_back(outStride[dim]);
+            }
+            rowStride.assign(gatherShape.size(), 1);
+            for (size_t d = gatherShape.size() - 1; d > 0; --d) {
+                rowStride[d - 1] = rowStride[d] * gatherShape[d];
+            }
+            JST_CHECK(rows.create(input.device(), DataType::CF32, {input.size() / n, n}));
         }
         return Result::SUCCESS;
     }
@@ -168,6 +204,15 @@ struct FftImplB200 : public FftImpl, public NativeCudaRuntimeContext, public Sch
             return Check(b200_fft_exec_real(plan, DevicePtr<float>(input), DevicePtr<void>(output), complexOutput ? 0 : 1, stream),
                          "FFT");
         }
+        if (!gatherShape.empty()) {
+            const int rank = static_cast<int>(gatherShape.size());
+            auto* scratch = DevicePtr<b200_cf32>(rows);
+            JST_CHECK(Check(b200_copy_strided(B200Ctx(), DevicePtr<b200_cf32>(input), scratch, 8, rank, gatherShape.data(),
+                                              inputStride.data(), rowStride.data(), stream), "FFT"));
+            JST_CHECK(Check(b200_fft_exec(plan, scratch, scratch, forward ? 1 : 0, stream), "FFT"));
+            return Check(b200_copy_strided(B200Ctx(), scratch, DevicePtr<b200_cf32>(output), 8, rank, gatherShape.data(),
+                                           rowStride.data(), outputStride.data(), stream), "FFT");
+        }
         return Check(b200_fft_exec(plan, DevicePtr<b200_cf32>(input), DevicePtr<b200_cf32>(output), forward ? 1 : 0,
                                    stream), "FFT");
     }
@@ -178,6 +223,8 @@ struct FftImplB200 : public FftImpl, public NativeCudaRuntimeContext, public Sch
     }
     b200_fft_plan* plan = nullptr;
     bool realInput = false;
+    Tensor rows;                                                   // [rows, n] gather scratch (other axes only)
+    std::vector<U64> gatherShape, inputStride, outputStride, rowStride;
 };
 JST_REGISTER_MODULE(FftImplB200, DeviceType::CUDA, RuntimeType::NATIVE, "b200");
 
@@ -583,6 +630,235 @@ struct FirFilterImplB200 : public Module::Impl, public DynamicConfig<FirFilter>,
     std::vector<b200_fir_plan*> plans;
 };
 JST_REGISTER_MODULE(FirFilterImplB200, DeviceType::CUDA, RuntimeType::NATIVE, "b200");
+
+// ---- the separate stages of the filter wiring: pad, unpad, fold, overlap_add, phase_correction --------------------
+// What the `filter` block (layouts the fused FIR does not take) and the `filter_engine` block wire between their FFTs,
+// src/domains/dsp/filter/block_impl.cc:350-582. pad, unpad, fold and overlap_add are not DISCONTIGUOUS: the reference
+// hands them contiguous inputs (src/module.cc:154-157), viewed here as [outer, axis, inner].
+namespace {
+
+bool RealOrComplex(const Tensor& tensor) {
+    return tensor.dtype() == DataType::F32 || tensor.dtype() == DataType::CF32;
+}
+
+void AxisView(const Shape& shape, const Index axis, U64& outer, U64& inner) {
+    outer = 1;
+    inner = 1;
+    for (Index d = 0; d < axis; ++d) outer *= shape[d];
+    for (Index d = axis + 1; d < shape.size(); ++d) inner *= shape[d];
+}
+
+}  // namespace
+
+// pad — src/domains/core/pad/module_impl_native_cpu.cc:75-142: the body is one strided copy, the zero tail a stride-0
+// copy of a zeroed element (a plain memset when there is a single outer slice).
+struct PadImplB200 : public PadImpl, public NativeCudaRuntimeContext, public Scheduler::Context {
+    Result create() final {
+        JST_CHECK(PadImpl::create());
+        if (!RealOrComplex(input)) {
+            JST_ERROR("[MODULE_PAD_B200] Unsupported data type '{}' (F32 and CF32 only).", input.dtype());
+            return Result::ERROR;
+        }
+        AxisView(input.shape(), resolvedAxis, outer, inner);
+        JST_CHECK(zero.create(input.device(), input.dtype(), {1}));    // zero-filled allocation
+        return Result::SUCCESS;
+    }
+    Result computeSubmit(const cudaStream_t& stream) override {
+        const int bytes = static_cast<int>(input.elementSize());
+        auto* out = DevicePtr<std::uint8_t>(output);
+        const U64 body = inputAxisSize * inner, row = outputAxisSize * inner, tail = size * inner;
+        const U64 shape[2] = {outer, body}, src[2] = {body, 1}, dst[2] = {row, 1};
+        JST_CHECK(Check(b200_copy_strided(B200Ctx(), DevicePtr<void>(input), out, bytes, 2, shape, src, dst, stream), "PAD"));
+        if (tail == 0) {
+            return Result::SUCCESS;
+        }
+        if (outer == 1) {
+            return Check(b200_memset(B200Ctx(), out + body * bytes, 0, tail * bytes, stream), "PAD");
+        }
+        const U64 tailShape[2] = {outer, tail}, zeroStride[2] = {0, 0};
+        return Check(b200_copy_strided(B200Ctx(), DevicePtr<void>(zero), out + body * bytes, bytes, 2, tailShape, zeroStride,
+                                       dst, stream), "PAD");
+    }
+    U64 outer = 1, inner = 1;
+    Tensor zero;
+};
+JST_REGISTER_MODULE(PadImplB200, DeviceType::CUDA, RuntimeType::NATIVE, "b200");
+
+// unpad — src/domains/core/unpad/module_impl_native_cpu.cc:75-142: body and tail, two strided copies.
+struct UnpadImplB200 : public UnpadImpl, public NativeCudaRuntimeContext, public Scheduler::Context {
+    Result create() final {
+        JST_CHECK(UnpadImpl::create());
+        if (!RealOrComplex(input)) {
+            JST_ERROR("[MODULE_UNPAD_B200] Unsupported data type '{}' (F32 and CF32 only).", input.dtype());
+            return Result::ERROR;
+        }
+        AxisView(input.shape(), resolvedAxis, outer, inner);
+        return Result::SUCCESS;
+    }
+    Result computeSubmit(const cudaStream_t& stream) override {
+        const int bytes = static_cast<int>(input.elementSize());
+        const auto* in = DevicePtr<std::uint8_t>(input);
+        const U64 row = inputAxisSize * inner, body = unpadAxisSize * inner, tail = size * inner;
+        if (body != 0) {
+            const U64 shape[2] = {outer, body}, src[2] = {row, 1}, dst[2] = {body, 1};
+            JST_CHECK(Check(b200_copy_strided(B200Ctx(), in, DevicePtr<void>(outputUnpadded), bytes, 2, shape, src, dst,
+                                              stream), "UNPAD"));
+        }
+        if (tail != 0) {
+            const U64 shape[2] = {outer, tail}, src[2] = {row, 1}, dst[2] = {tail, 1};
+            JST_CHECK(Check(b200_copy_strided(B200Ctx(), in + body * bytes, DevicePtr<void>(outputPad), bytes, 2, shape, src,
+                                              dst, stream), "UNPAD"));
+        }
+        return Result::SUCCESS;
+    }
+    U64 outer = 1, inner = 1;
+};
+JST_REGISTER_MODULE(UnpadImplB200, DeviceType::CUDA, RuntimeType::NATIVE, "b200");
+
+// fold — b200_fold. The per-channel offsets (input attribute "channelOffsets") go to the device once, when the module
+// initialises.
+struct FoldImplB200 : public FoldImpl, public NativeCudaRuntimeContext, public Scheduler::Context {
+    Result create() final {
+        JST_CHECK(FoldImpl::create());
+        if (!RealOrComplex(input)) {
+            JST_ERROR("[MODULE_FOLD_B200] Unsupported input data type: {}.", input.dtype());
+            return Result::ERROR;
+        }
+        AxisView(input.shape(), resolvedAxis, outer, inner);
+        channelInner = 1;
+        if (!channelOffsets.empty()) {
+            for (Index d = *channelAxis + 1; d < output.rank(); ++d) channelInner *= output.shape(d);
+        }
+        return Result::SUCCESS;
+    }
+    Result computeInitialize() override {
+        if (channelOffsets.empty()) {
+            return Result::SUCCESS;
+        }
+        const U64 bytes = channelOffsets.size() * sizeof(U64);
+        JST_CHECK(Check(b200_malloc(B200Ctx(), bytes, &offsetsDevice), "FOLD"));
+        JST_CHECK(Check(b200_memcpy(B200Ctx(), offsetsDevice, channelOffsets.data(), bytes, 0, nullptr), "FOLD"));
+        return Check(b200_stream_synchronize(B200Ctx(), nullptr), "FOLD");
+    }
+    Result computeSubmit(const cudaStream_t& stream) override {
+        return Check(b200_fold(B200Ctx(), DevicePtr<void>(input), DevicePtr<void>(output),
+                               input.dtype() == DataType::CF32 ? 1 : 0, outer, input.shape(resolvedAxis), inner, size,
+                               offset, static_cast<const uint64_t*>(offsetsDevice), channelOffsets.size(), channelInner,
+                               stream), "FOLD");
+    }
+    Result computeDeinitialize() override {
+        const auto result = Check(b200_free(B200Ctx(), offsetsDevice), "FOLD");
+        offsetsDevice = nullptr;
+        return result;
+    }
+    U64 outer = 1, inner = 1, channelInner = 1;
+    void* offsetsDevice = nullptr;
+};
+JST_REGISTER_MODULE(FoldImplB200, DeviceType::CUDA, RuntimeType::NATIVE, "b200");
+
+// overlap_add — b200_overlap_add. previousOverlap is the reference's own module tensor, allocated on the device (zero-
+// filled) and carried there. create() repeats OverlapAddImpl::create (module_impl.cc:129-151) except its host
+// std::memset of that tensor, which a device allocation does not allow.
+struct OverlapAddImplB200 : public OverlapAddImpl, public NativeCudaRuntimeContext, public Scheduler::Context {
+    Result create() final {
+        inputBuffer = validatedInputBuffer;
+        inputOverlap = validatedInputOverlap;
+        batchAxis = validatedBatchAxis;
+        if (!RealOrComplex(inputBuffer) || inputOverlap.dtype() != inputBuffer.dtype()) {
+            JST_ERROR("[MODULE_OVERLAP_ADD_B200] Buffer and overlap must both be F32 or both CF32.");
+            return Result::ERROR;
+        }
+        JST_CHECK(output.create(inputBuffer.device(), inputBuffer.dtype(), inputBuffer.shape()));
+        JST_CHECK(output.propagateAttributes(inputBuffer));
+        JST_CHECK(previousOverlap.create(inputBuffer.device(), inputBuffer.dtype(), validatedPreviousOverlapShape));
+        outputs()["buffer"].produced(name(), "buffer", output);
+
+        SignalAxes axes;
+        JST_CHECK(ResolveSignalAxes(inputBuffer, axes));
+        sampleAxis = *axes.sample;
+        AxisView(inputBuffer.shape(), sampleAxis, outer, inner);
+        batches = batchAxis ? inputOverlap.shape(*batchAxis) : 1;
+        batchStride = inputOverlap.size();
+        if (batchAxis) {
+            U64 ignored = 1;
+            AxisView(inputOverlap.shape(), *batchAxis, ignored, batchStride);
+        }
+        return Result::SUCCESS;
+    }
+    Result computeSubmit(const cudaStream_t& stream) override {
+        return Check(b200_overlap_add(B200Ctx(), DevicePtr<void>(inputBuffer), DevicePtr<void>(inputOverlap),
+                                      DevicePtr<void>(output), DevicePtr<void>(previousOverlap),
+                                      inputBuffer.dtype() == DataType::CF32 ? 1 : 0, outer, inputBuffer.shape(sampleAxis),
+                                      inputOverlap.shape(sampleAxis), inner, batches, batchStride, stream),
+                     "OVERLAP_ADD");
+    }
+    Index sampleAxis = 0;
+    U64 outer = 1, inner = 1, batches = 1, batchStride = 1;
+};
+JST_REGISTER_MODULE(OverlapAddImplB200, DeviceType::CUDA, RuntimeType::NATIVE, "b200");
+
+// phase_correction — b200_phase_correction. The per-channel phases advance by host arithmetic that does not depend on
+// the data, kept here in F64 exactly as PhaseCorrectionImplNativeCpu keeps them (module_impl_native_cpu.cc:55-115).
+// The module is DISCONTIGUOUS: a strided input is gathered into a contiguous scratch first.
+struct PhaseCorrectionImplB200 : public PhaseCorrectionImpl, public NativeCudaRuntimeContext, public Scheduler::Context {
+    Result create() final {
+        JST_CHECK(PhaseCorrectionImpl::create());
+        if (input.dtype() != DataType::CF32) {
+            JST_ERROR("[MODULE_PHASE_CORRECTION_B200] Input must be CF32.");
+            return Result::ERROR;
+        }
+        U64 ignored = 1;
+        batchCount = batchAxis ? input.shape(*batchAxis) : 1;
+        batchInner = 1;
+        if (batchAxis) AxisView(input.shape(), *batchAxis, ignored, batchInner);
+        channelCount = channelAxis ? input.shape(*channelAxis) : 1;
+        channelInner = 1;
+        if (channelAxis) AxisView(input.shape(), *channelAxis, ignored, channelInner);
+        if (channelCount > B200_PHASE_CORRECTION_MAX_CHANNELS) {
+            JST_ERROR("[MODULE_PHASE_CORRECTION_B200] {} channels exceed the supported {}.", channelCount,
+                      B200_PHASE_CORRECTION_MAX_CHANNELS);
+            return Result::ERROR;
+        }
+        phases.assign(channelCount, 0.0);
+        wrappedPhaseIncrements.resize(channelCount);
+        for (U64 channel = 0; channel < channelCount; ++channel) {
+            const F64 increment = channelPhaseIncrements.empty() ? phaseIncrement : channelPhaseIncrements[channel];
+            wrappedPhaseIncrements[channel] = std::remainder(increment, 2.0 * JST_PI);
+        }
+        gathered = Tensor();
+        if (!input.contiguous()) {
+            if (input.rank() > 8) {
+                JST_ERROR("[MODULE_PHASE_CORRECTION_B200] Rank {} exceeds the supported 8.", input.rank());
+                return Result::ERROR;
+            }
+            JST_CHECK(gathered.create(input.device(), DataType::CF32, input.shape()));
+        }
+        return Result::SUCCESS;
+    }
+    Result computeSubmit(const cudaStream_t& stream) override {
+        const b200_cf32* in = DevicePtr<b200_cf32>(input);
+        if (gathered.size() != 0) {
+            const std::vector<U64> shape(input.shape().begin(), input.shape().end());
+            const std::vector<U64> src(input.stride().begin(), input.stride().end());
+            const std::vector<U64> dst(gathered.stride().begin(), gathered.stride().end());
+            JST_CHECK(Check(b200_copy_strided(B200Ctx(), in, DevicePtr<b200_cf32>(gathered), 8, static_cast<int>(input.rank()),
+                                              shape.data(), src.data(), dst.data(), stream), "PHASE_CORRECTION"));
+            in = DevicePtr<b200_cf32>(gathered);
+        }
+        JST_CHECK(Check(b200_phase_correction(B200Ctx(), in, DevicePtr<b200_cf32>(output), output.size(), batchCount,
+                                              batchInner, channelCount, channelInner, phases.data(),
+                                              wrappedPhaseIncrements.data(), stream), "PHASE_CORRECTION"));
+        for (U64 channel = 0; channel < channelCount; ++channel) {
+            phases[channel] = std::remainder(
+                phases[channel] + wrappedPhaseIncrements[channel] * static_cast<F64>(batchCount), 2.0 * JST_PI);
+        }
+        return Result::SUCCESS;
+    }
+    U64 batchCount = 1, batchInner = 1, channelCount = 1, channelInner = 1;
+    std::vector<F64> phases, wrappedPhaseIncrements;
+    Tensor gathered;
+};
+JST_REGISTER_MODULE(PhaseCorrectionImplB200, DeviceType::CUDA, RuntimeType::NATIVE, "b200");
 
 // ---- lineplot / waterfall: the consumers right after the chain (SURVEY.md §8 f1) --------------------------------
 // validate / create / reconfigure / present are the reference's LineplotImpl / WaterfallImpl; computeSubmit replaces
