@@ -9,10 +9,12 @@
 // A CTA works on a block of THREADS*16 samples = G = BLOCK/N consecutive rows landed by ONE bulk TMA copy into
 // a 2-deep ring; passes ping-pong between an exchange buffer X1 and the row's own stage buffer, both addressed
 // through pad(a) = a + a/16 (one 8-byte pad per 16 elements), which makes every exchange store conflict-free
-// (tests/test_index_algebra.py) — so there is exactly one __syncthreads per pass boundary and no WAR barrier:
-// X1 is rewritten only after the barrier that follows its last read, and the stage buffer is refilled by TMA
-// only after the next block's first barrier. Twiddles W^{k t} are thread-constant per (pass, butterfly):
-// stored powers w^1..w^3, w^4, w^8, w^12 from an F64-evaluated table.
+// (tests/test_index_algebra.py) — with one __syncthreads per pass boundary. A CTA loops over blocks, and a buffer
+// is rewritten only after a barrier that follows its last read: the next block's pass 0 rewrites X1 after a pass or
+// R2C unpack barrier, or, for 2 and 4 register passes, after one at the end of the block (a __syncwarp for the
+// warp-local rows of 2 passes); the stage buffer is refilled by TMA only after the next block's first barrier.
+// Twiddles W^{k t} are thread-constant per (pass, butterfly): stored powers w^1..w^3, w^4, w^8, w^12 from an
+// F64-evaluated table.
 #pragma once
 
 #include "fft4096.cuh"
@@ -425,6 +427,15 @@ __global__ void __launch_bounds__(radix_threads(LOG2N), 1)
                     stg_stream_f1(out + lt + b1 * T + t1 * NS_LAST, r.y);
                 }
             }
+        }
+        // With 2 or 4 passes the last pass read X1 across the row's threads and no barrier has followed (R2C's unpack
+        // has one): order those reads before the next block's pass 0 rewrites X1. Rows of 2-pass lengths are warp-local.
+        if constexpr (MODE != MODE_R2C && PASSES == 4) {
+            __syncthreads();
+        }
+        if constexpr (MODE != MODE_R2C && PASSES == 2) {
+            static_assert(32 % T == 0, "a row of a two-pass length must lie within one warp");
+            __syncwarp();
         }
 
         refill_stage = stage;

@@ -1,6 +1,12 @@
 """The index algebra of the two FFT kernels, emulated in numpy (F64) against np.fft: the 16x16x16 three-pass
 scheme of fft4096_kernel (including both shared-memory exchange layouts) and the generic Stockham passes."""
+import os
+import re
+from collections import defaultdict
+
 import numpy as np
+
+CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "cyberether_b200", "csrc")
 
 
 def W(n, e):
@@ -189,7 +195,6 @@ def test_fft_radix_kernel_padded_stockham_scheme():
     """fft_radix_kernel (16 <= N <= 8192): block of THREADS*16 samples, passes ping-pong between the exchange
     buffer and the stage buffer through pad(a) = a + a/16; checks the result and that every exchange store of a
     half-warp hits 16 distinct 8-byte bank pairs."""
-    from collections import defaultdict
     pad = lambda a: a + (a >> 4)
     for log2n in range(4, 14):
         n, rad = 1 << log2n, _radices(log2n)
@@ -229,6 +234,190 @@ def test_fft_radix_kernel_padded_stockham_scheme():
             ns *= r
         want = np.fft.fft(x.reshape(rows, n), axis=1).reshape(-1)
         assert np.abs(out - want).max() < 1e-9 * n, log2n
+
+
+_KERNEL_MODES = {"MODE_C2C": 0, "MODE_AMP": 1, "MODE_AMP_RANGE": 2, "MODE_C2C_T": 3, "MODE_R2C": 4}   # fft_common.cuh
+
+
+def _radix_kernel_code():
+    """fft_radix_kernel's source from its signature on, comments removed, and the part from its epilogue on."""
+    with open(os.path.join(CSRC, "fft_radix.cuh")) as f:
+        text = f.read()
+    kernel = text[text.index("fft_radix_kernel(const FftParams p)"):]
+    strip = lambda s: re.sub(r"//[^\n]*", "", s)
+    return strip(kernel), strip(kernel[kernel.index("// ---- epilogue"):])
+
+
+def _radix_block_end(epilogue):
+    """The kernel code between a block's epilogue (an if / else chain) and the ring-index update that ends the block."""
+    i = epilogue.index("{")
+    while True:
+        depth = 0
+        for j in range(i, len(epilogue)):
+            depth += {"{": 1, "}": -1}.get(epilogue[j], 0)
+            if depth == 0:
+                break
+        rest = epilogue[j + 1:]
+        if not rest.lstrip().startswith("else"):
+            return rest[:rest.index("refill_stage = stage;")]
+        i = j + 1 + rest.index("{")
+
+
+def _radix_block_end_fences(tail, mode, log2n):
+    """The __syncthreads / __syncwarp statements of the block end, with their `if constexpr` guards evaluated for
+    (mode, log2n)."""
+    names = dict(_KERNEL_MODES, MODE=_KERNEL_MODES[mode], LOG2N=log2n, N=1 << log2n, T=(1 << log2n) // 16,
+                 PASSES=(log2n + 3) // 4)
+    fences = []
+    for m in re.finditer(r"if constexpr \(([^{}]*)\)\s*\{([^{}]*)\}|(__syncthreads|__syncwarp)\(\)", tail):
+        if m.group(3):
+            fences.append(m.group(3))
+        elif eval(m.group(1).replace("&&", " and ").replace("||", " or "), {"__builtins__": {}}, names):
+            fences += re.findall(r"__syncthreads|__syncwarp", m.group(2))
+    return fences
+
+
+_RADIX_SYNCTHREADS_IN_BODY = 7      # the __syncthreads statements of the kernel outside the block-end fences
+
+
+def _radix_kernel_schedule(log2n, mode, block_end_fences, blocks=3, my_blocks=5):
+    """Program order of every thread of one fft_radix_kernel<log2n, mode> CTA over its first `blocks` blocks (of
+    `my_blocks`): ("r" | "w", buffer, element) shared-memory accesses with buffer "stage0", "stage1" or "x1", ("sync",)
+    for __syncthreads, ("syncwarp",), ("wait", block) for mbar_wait on the block's stage and ("tma", stage, block) for a
+    bulk copy of `block` into `stage` issued by thread 0."""
+    n, rad = 1 << log2n, _radices(log2n)
+    threads, t_per_row, passes = max(256, n // 16), n // 16, len(rad)
+    pad = lambda a: a + (a >> 4)
+    program = []
+    for tid in range(threads):
+        ev, (g, lt) = [], divmod(tid, t_per_row)
+        row = g * n
+        issued = 0
+
+        def refill(stage):
+            nonlocal issued
+            if issued < my_blocks:
+                if tid == 0:
+                    ev.append(("tma", stage, issued))
+                issued += 1
+
+        ev.append(("sync",))                                  # after the mbarrier init
+        for s in range(2):
+            refill(s)
+        stage, refill_stage = 0, 0
+        for i in range(blocks):
+            sb = f"stage{stage}"
+            ev.append(("wait", i))
+            ev += [("r", sb, row + lt + t * t_per_row) for t in range(16)]          # pass 0 reads the linear TMA block
+            if passes == 1:
+                ev.append(("sync",))
+                refill(stage)
+            else:
+                ev += [("w", "x1", pad(row + lt * 16 + t)) for t in range(16)]
+                ev.append(("sync",))
+                if i >= 1:
+                    refill(refill_stage)
+                r1 = rad[1]
+                for b in range(16 // r1):                     # pass 1 reads X1, writes the stage buffer unless last
+                    j = lt + b * t_per_row
+                    k = j & 15
+                    ev += [("r", "x1", pad(row + j + t * (n // r1))) for t in range(r1)]
+                    if passes > 2:
+                        ev += [("w", sb, pad(row + (j - k) * r1 + k + t * 16)) for t in range(r1)]
+            if passes > 2:
+                ev.append(("sync",))
+                r2 = rad[2]
+                for b in range(16 // r2):                     # pass 2 reads the stage buffer, writes X1 unless last
+                    j = lt + b * t_per_row
+                    k = j & 255
+                    ev += [("r", sb, pad(row + j + t * (n // r2))) for t in range(r2)]
+                    if passes > 3:
+                        ev += [("w", "x1", pad(row + (j - k) * r2 + k + t * 256)) for t in range(r2)]
+            if passes > 3:
+                ev.append(("sync",))
+                for b in range(8):                            # pass 3 (radix 2) reads X1
+                    j = lt + b * t_per_row
+                    ev += [("r", "x1", pad(row + j)), ("r", "x1", pad(row + j + n // 2))]
+            if mode == "MODE_R2C":                            # Z through the buffer the last pass did not read
+                rl = rad[-1]
+                zbuf = "x1" if passes % 2 == 1 else sb
+                ev += [("w", zbuf, row + lt + b * t_per_row + t * (n // rl)) for b in range(16 // rl) for t in range(rl)]
+                ev.append(("sync",))
+                for j in range(9):
+                    k = lt + j * t_per_row
+                    if j == 8 and lt != 0:
+                        break
+                    ev += [("r", zbuf, row)] if k == 0 else [("r", zbuf, row + k), ("r", zbuf, row + n - k)]
+                if passes % 2 == 1:
+                    ev.append(("sync",))
+            # the C2C, C2C_T and spectral epilogues go from registers to global memory
+            ev += [("sync",) if f == "__syncthreads" else ("syncwarp",) for f in block_end_fences]
+            refill_stage, stage = stage, stage ^ 1
+        program.append(ev)
+    return program
+
+
+def _schedule_races(program):
+    """Unordered pairs in a schedule. Generic accesses: different threads, the same element, at least one write, no
+    __syncthreads between them, and (same warp) no __syncwarp between them. A bulk copy into a stage is in flight from
+    its issue by thread 0 until each thread's wait for that block; any generic access to the stage meanwhile races."""
+    by_element = defaultdict(list)
+    stage_access, tma, waits = [], [], {}
+    for tid, ev in enumerate(program):
+        interval = epoch = 0
+        for pos, e in enumerate(ev):
+            if e[0] == "sync":
+                interval += 1
+                epoch += 1
+            elif e[0] == "syncwarp":
+                epoch += 1
+            elif e[0] == "wait":
+                waits[tid, e[1]] = pos
+            elif e[0] == "tma":
+                tma.append((e[1], e[2], interval, pos))
+            else:
+                by_element[interval, e[1], e[2]].append((tid, e[0] == "w", epoch))
+                if e[1] != "x1":
+                    stage_access.append((tid, interval, pos, int(e[1][-1])))
+    races = []
+    for (interval, buf, elem), acc in by_element.items():
+        if len(acc) < 2 or not any(w for _, w, _ in acc):
+            continue
+        for a, (ta, wa, ea) in enumerate(acc):
+            for tb, wb, eb in acc[a + 1:]:
+                if ta != tb and (wa or wb) and not (ta // 32 == tb // 32 and ea != eb):
+                    races.append(f"{buf}[{elem}]: threads {ta} and {tb} after barrier {interval}")
+    tid, interval, pos, stage = np.array(stage_access).T
+    for s, block, issue_interval, issue_pos in tma:
+        wait_pos = np.array([waits.get((t, block), 1 << 62) for t in range(len(program))])
+        after_issue = (interval > issue_interval) | ((interval == issue_interval) & ((tid != 0) | (pos > issue_pos)))
+        hit = (stage == s) & after_issue & (pos < wait_pos[tid])
+        if hit.any():
+            races.append(f"stage{s} refill with block {block}: thread {tid[hit][0]} touches it while in flight")
+    return races
+
+
+def test_fft_radix_kernel_schedule_is_race_free_across_consecutive_blocks():
+    """fft_radix_kernel is persistent: a CTA runs blocks first, first + gridDim.x, ... whenever the batch exceeds the grid,
+    so one block's last exchange reads meet the next block's first exchange stores, and the two-stage TMA ring wraps. For
+    every length and mode family (C2C / C2C_T, amplitude / range, R2C) the model below replays three consecutive blocks of
+    one CTA and checks that every pair of shared-memory accesses that could race is ordered.
+
+    The model is a hand restatement of fft_radix.cuh: a change to the kernel's shared-memory schedule must change the
+    model too. Two parts are read from the kernel source instead: the fences between a block's epilogue and the next
+    block (so the test checks the kernel as it is), and the number of __syncthreads statements, which must match the
+    restatement."""
+    code, epilogue = _radix_kernel_code()
+    tail = _radix_block_end(epilogue)
+    failures = []
+    for mode in ("MODE_C2C", "MODE_AMP_RANGE", "MODE_R2C"):
+        for log2n in range(5 if mode == "MODE_R2C" else 4, 14):
+            fences = _radix_block_end_fences(tail, mode, log2n)
+            races = _schedule_races(_radix_kernel_schedule(log2n, mode, fences))
+            if races:
+                failures.append(f"LOG2N={log2n} {mode}: {len(races)} races, e.g. {races[0]}")
+    assert not failures, "\n".join(failures)
+    assert code.count("__syncthreads()") == _RADIX_SYNCTHREADS_IN_BODY + tail.count("__syncthreads()")
 
 
 def test_fm_nco_wrap_identity_exhaustive():
