@@ -84,6 +84,7 @@ SIGNATURES = {
     "b200_chain_plan_variant": (ctypes.c_char_p, [c_vp]),
     "b200_filter_taps_host": (c_int, [ctypes.c_double, ctypes.c_double, P(ctypes.c_double), c_u64, c_u64, c_vp]),
     "b200_fir_plan_create": (c_int, [c_vp, c_vp, c_u64, c_u64, c_u64, P(c_vp)]),
+    "b200_fir_plan_variant": (ctypes.c_char_p, [c_vp]),
     "b200_fir_plan_set_translation": (c_int, [c_vp, c_u64, P(ctypes.c_int64)]),
     "b200_fir_exec": (c_int, [c_vp, c_vp, c_vp, c_u64, c_u64, c_vp]),
     "b200_fir_reset": (c_int, [c_vp, c_vp]),

@@ -18,7 +18,9 @@
 #include <algorithm>
 #include <cmath>
 #include <complex>
+#include <cstdio>
 #include <cstdlib>
+#include <string>
 #include <type_traits>
 #include <vector>
 
@@ -350,6 +352,7 @@ struct b200_fir_plan {
     uint32_t pair_lp_pad = 0, pair_hpad = 0, pair_threads = 0, pair_qt = 0, pair_pitch = 0;
     size_t pair_smem = 0;
     std::vector<float> pair_taps_host;  // [heads][R/2][lp_pad] x (h[2c], h[2c-1])
+    std::string variant;                // b200_fir_plan_variant
     float* taps_dev;
     float2* hist[2];
     int cur;
@@ -444,6 +447,21 @@ static FirGeometry fir_geometry(const uint32_t L, const uint32_t R, const uint32
         }
     }
     return g;
+}
+
+// Most CTAs one exec launches for a tile of `smem` bytes: up to eight per SM, as many as share its shared memory.
+static uint64_t fir_cta_cap(const b200_fir_plan* pl, const size_t smem) {
+    const uint64_t per_sm = std::max<uint64_t>(1, std::min<uint64_t>(8, (220 * 1024) / (smem + 1024)));
+    return static_cast<uint64_t>(pl->ctx->sms) * per_sm;
+}
+
+static std::string fir_form_name(const b200_fir_plan* pl, const char* form, const int ob, const uint32_t threads,
+                                 const bool const_taps, const uint32_t qt, const size_t smem) {
+    char buf[160];
+    snprintf(buf, sizeof(buf), "%s OB=%d threads=%u taps=%s %s qt=%u ctas=%llu", form, ob, threads,
+             const_taps ? "const" : "shared", pl->real_taps ? "real" : "complex", qt,
+             static_cast<unsigned long long>(fir_cta_cap(pl, smem)));
+    return buf;
 }
 
 template <int OB>
@@ -596,6 +614,10 @@ int b200_fir_plan_create(b200_ctx* ctx, const b200_cf32* taps_host, uint64_t nta
             pl->pair_taps_host = pair;
         }
     }
+    pl->variant = fir_form_name(pl, "sample", pl->ob, pl->threads, pl->const_taps, pl->qt, pl->smem);
+    if (pl->pair_ok) {
+        pl->variant += "; " + fir_form_name(pl, "pair", pl->pair_ob, pl->pair_threads, true, pl->pair_qt, pl->pair_smem);
+    }
     void* dev = nullptr;
     if (b200_malloc(ctx, host.size() * sizeof(float), &dev) != B200_SUCCESS) {
         delete pl;
@@ -620,6 +642,8 @@ int b200_fir_plan_create(b200_ctx* ctx, const b200_cf32* taps_host, uint64_t nta
     *plan = pl;
     return B200_SUCCESS;
 }
+
+const char* b200_fir_plan_variant(const b200_fir_plan* plan) { return plan ? plan->variant.c_str() : ""; }
 
 int b200_fir_plan_set_translation(b200_fir_plan* plan, uint64_t frame_len, const int64_t* center_bins) {
     B200_REQUIRE(plan && center_bins, "b200_fir_plan_set_translation: null argument");
@@ -782,8 +806,7 @@ int b200_fir_exec(b200_fir_plan* plan, const b200_cf32* x, b200_cf32* y, uint64_
         q.lp = (q.L + q.R - 1) / q.R;
         q.lp_thr = q.L - (q.lp - 1) * q.R;
         const uint64_t tiles = (q.n_out + q.qt - 1) / q.qt;
-        const uint64_t per_sm = std::max<uint64_t>(1, std::min<uint64_t>(8, (220 * 1024) / (plan->pair_smem + 1024)));
-        const unsigned grid = static_cast<unsigned>(std::min<uint64_t>(tiles, static_cast<uint64_t>(plan->ctx->sms) * per_sm));
+        const unsigned grid = static_cast<unsigned>(std::min<uint64_t>(tiles, fir_cta_cap(plan, plan->pair_smem)));
         switch (plan->pair_ob) {
             case 7: rc = fir_launch_pair<7>(plan, q, grid, s); break;
             case 5: rc = fir_launch_pair<5>(plan, q, grid, s); break;
@@ -792,9 +815,7 @@ int b200_fir_exec(b200_fir_plan* plan, const b200_cf32* x, b200_cf32* y, uint64_
         }
     } else {
         const uint64_t tiles = (p.n_out + p.qt - 1) / p.qt;
-        const uint64_t per_sm = std::max<uint64_t>(1, std::min<uint64_t>(8, (220 * 1024) / (plan->smem + 1024)));
-        const uint64_t cap = static_cast<uint64_t>(plan->ctx->sms) * per_sm;
-        const unsigned grid = static_cast<unsigned>(std::min<uint64_t>(tiles, cap));
+        const unsigned grid = static_cast<unsigned>(std::min<uint64_t>(tiles, fir_cta_cap(plan, plan->smem)));
         switch (plan->ob) {
             case 7: rc = fir_launch<7>(plan, p, grid, s); break;
             case 5: rc = fir_launch<5>(plan, p, grid, s); break;

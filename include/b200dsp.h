@@ -323,6 +323,12 @@ int b200_filter_taps_host(double sample_rate, double bandwidth, const double* ce
  * output tail in overlap_add, module_impl_native_cpu.cc:155-198); b200_fir_reset zeroes it. */
 int b200_fir_plan_create(b200_ctx* ctx, const b200_cf32* taps_host, uint64_t ntaps, uint64_t heads,
                          uint64_t decimation, b200_fir_plan** plan);
+/* The kernel forms exec() can launch for this plan (for logs / tests): the 8-byte sample form, and the 16-byte chunk-pair
+ * form when the plan has one, e.g. "sample OB=7 threads=64 taps=const real qt=448 ctas=792; pair OB=5 threads=128
+ * taps=const real qt=640 ctas=528". OB = outputs per thread, qt = outputs per tile, taps = tap table in the kernel
+ * parameters or in shared memory, ctas = most CTAs one launch uses. A call takes the pair form only when its input is
+ * 16-byte aligned and of even length, so the string says what is eligible, not what a given call ran. */
+const char* b200_fir_plan_variant(const b200_fir_plan* plan);
 /* Frequency-translating heads = the block's fold offsets + phase_correction module (block_impl.cc:118-160,
  * 519-532; src/domains/dsp/fold/module_impl_native_cpu.cc:130-147; src/domains/dsp/phase_correction/
  * module_impl_native_cpu.cc:81-115): head h is shifted down by center_bins[h] bins of the block's M-point spectrum

@@ -182,6 +182,119 @@ def test_fir_chunk_pair_form():
             assert abs(acc - want) < 1e-9, (L, R, o)
 
 
+def _fir_thread_loop(planes, taps, R, C, ob, o0, hpad, lp_pad, mul):
+    """One thread of fir_decim_kernel as written: outputs o0 .. o0 + OB - 1 of a tile from `planes` (rows of staged
+    elements per plane, None where nothing is staged) and the host's re-ordered tap table taps[plane][slot] (padded
+    slots hold a poison value). Window element i lives in w[(i - s) mod OB]; after tap step s, w[(OB - 1 - s) mod OB]
+    takes xq[-s - 1]; the OB-wide blocks run `full` taps, the tail loop `rem`; plane p holds lp_plane taps, from lp_thr
+    without a division. C = taps in element units (L, or (L + 1) / 2 chunk-taps)."""
+    lp = -(-C // R)
+    lp_thr = C - (lp - 1) * R
+    acc = [0] * ob
+    for plane in range(R):
+        d = hpad if plane == 0 else hpad - 1
+        row = o0 + d                                        # xp = planes[plane] + o0 + d
+        w = [planes[plane][row + i] for i in range(ob)]
+        kp0 = 0 if plane == 0 else R - plane
+        lp_plane = lp - (1 if kp0 >= lp_thr else 0)
+        full = lp_plane // ob * ob
+        slot = 0
+
+        def tap_step(s):
+            h = taps[plane][slot + s]
+            for i in range(ob):
+                v = w[(i - s) % ob]
+                assert v is not None, "the loop read an element the tile did not stage"
+                acc[i] += mul(h, v)
+            assert row - s - 1 >= 0, "the slide reads below the tile"
+            w[(ob - 1 - s) % ob] = planes[plane][row - s - 1]
+        for _ in range(0, full, ob):
+            for s in range(ob):
+                tap_step(s)
+            row -= ob
+            slot += ob
+        for s in range(ob - 1):
+            if s < lp_plane - full:
+                tap_step(s)
+        assert slot + lp_plane - full <= lp_pad
+    return acc
+
+
+def _fir_tile(elements, R, qt, hpad):
+    """Stage a tile starting at output q0 = hpad (stream index j0 = 0) the way the kernel does: element i -> plane
+    i mod R, row i div R, for the span of (qt - 1) R + hpad R + 1 elements."""
+    span = (qt - 1) * R + hpad * R + 1
+    planes = [[None] * (qt + hpad + 1) for _ in range(R)]
+    for i in range(span):
+        planes[i % R][i // R] = elements[i]
+    return planes
+
+
+def _fir_table(g, R, C, lp_pad, poison):
+    """Host re-ordering: plane p, slot m <- g[kp0 + m R], kp0 = (R - p) mod R; poison beyond C."""
+    return [[g[(R - p) % R + m * R] if (R - p) % R + m * R < C else poison for m in range(lp_pad)] for p in range(R)]
+
+
+def test_fir_thread_tap_loop_equals_direct_convolution():
+    """The thread loop of fir_decim_kernel (window rotation, slide, full / rem split, lp_plane from lp_thr) replayed
+    with integers for OB = 1, 3, 5, 7, every L <= 70 and R <= 20 (L < R, L = k R, L = k R + 1 among them), for the
+    first and the last thread of a tile: equal to y[q] = sum_k h[k] x[q R - k]. Padded tap slots hold a poison value,
+    so a loop that multiplies one instead of skipping it fails; reads of unstaged rows fail too."""
+    rng = np.random.default_rng(11)
+    poison = 10 ** 9
+    for ob in (1, 3, 5, 7):
+        threads = 2
+        qt = threads * ob
+        for R in range(1, 21):
+            for L in range(1, 71):
+                lp = -(-L // R)
+                lp_pad = -(-lp // ob) * ob
+                hpad = lp_pad + 1
+                h = [int(v) for v in rng.integers(1, 9, L) * rng.choice([-1, 1], L)]
+                x = [int(v) for v in rng.integers(1, 9, (qt + hpad) * R) * rng.choice([-1, 1], (qt + hpad) * R)]
+                planes = _fir_tile(x, R, qt, hpad)
+                table = _fir_table(h, R, L, lp_pad, poison)
+                for t in range(threads):
+                    got = _fir_thread_loop(planes, table, R, L, ob, t * ob, hpad, lp_pad, lambda a, b: a * b)
+                    for i in range(ob):
+                        q = hpad + t * ob + i
+                        want = sum(h[k] * x[q * R - k] for k in range(L))
+                        assert got[i] == want, (ob, L, R, t, i)
+
+
+def test_fir_pair_thread_tap_loop_equals_direct_convolution():
+    """The same loop in the chunk-pair form: elements are chunks (x[2n], x[2n+1]), decimation R / 2, chunk-taps
+    g[c] = (h[2c], h[2c-1]) with h[-1] = 0, for odd L <= 69 and even R <= 20 (complex integer taps and samples)."""
+    rng = np.random.default_rng(12)
+    poison = (10 ** 9, 10 ** 9)
+
+    def rnd(n):
+        return [complex(a, b) for a, b in rng.integers(1, 9, (n, 2)) * rng.choice([-1, 1], (n, 2))]
+    for ob in (1, 3, 5, 7):
+        threads = 2
+        qt = threads * ob
+        for R in range(2, 21, 2):
+            R2 = R // 2
+            for L in range(1, 70, 2):
+                C = (L + 1) // 2
+                lp = -(-C // R2)
+                lp_pad = -(-lp // ob) * ob
+                hpad = lp_pad + 1
+                h = rnd(L)
+                x = rnd((qt + hpad) * R)
+                g = [(h[2 * c], h[2 * c - 1] if c > 0 else 0) for c in range(C)]
+                chunks = [(x[2 * n], x[2 * n + 1]) for n in range(len(x) // 2)]
+                planes = _fir_tile(chunks, R2, qt, hpad)
+                table = _fir_table(g, R2, C, lp_pad, poison)
+                for t in range(threads):
+                    got = _fir_thread_loop(planes, table, R2, C, ob, t * ob, hpad, lp_pad,
+                                           lambda gc, v: gc[0] * v[0] + gc[1] * v[1])
+                    for i in range(ob):
+                        q = hpad + t * ob + i
+                        want = sum(h[k] * x[q * R - k] for k in range(L))
+                        assert got[i] == want, (ob, L, R, t, i)
+
+
 def _radices(log2n):
     rem, out = 1 << log2n, []
     while rem > 1:
