@@ -98,6 +98,7 @@ SIGNATURES = {
     "b200_fm_reset": (c_int, [c_vp, c_vp]),
     "b200_fm_plan_destroy": (c_int, [c_vp]),
     "b200_fm_nco_phases_host": (c_int, [c_f32, c_u64, c_u64, c_vp, P(c_u64), P(c_u64)]),
+    "b200_fm_nco_phases": (c_int, [c_vp, c_u64, c_u64, c_vp, c_vp]),
 }
 
 _lib = None

@@ -63,7 +63,8 @@ __device__ __forceinline__ float discriminate(const float2 p, const float2 c, co
 // 2048 consecutive samples of one row (frame, lane), 8 samples per thread:
 //   1. 16-byte loads, d[k] in registers (the reference's rounding sequence + atan2f);
 //   2. each thread folds its 8 samples into the affine map y -> g y + o of the recurrence (zero-state response o in
-//      the reference's operation order, g = (1-alpha)^#finite), a warp-shuffle + shared-memory scan composes them;
+//      the reference's operation order, g = (1-alpha)^#finite, carried as the count #finite), a warp-shuffle +
+//      shared-memory scan composes them;
 //   3. the tile publishes its aggregate map, warp 0 looks back over the predecessor tiles of the same lane (tiles are
 //      numbered time-major, lanes innermost: predecessor = id - lanes) combining aggregates until it meets a tile whose
 //      inclusive carry is known, publishes its own carry, and
@@ -75,7 +76,8 @@ constexpr int kFmPerThread = 8;
 constexpr int kFmTile = kFmTileThreads * kFmPerThread;
 
 // Two self-validating 64-bit words per tile (64-bit accesses are single-copy atomic, so no fence is needed):
-//   a = (epoch << 2 | state) << 32 | bits(g or y)      state 1: aggregate map (g, o) published, 2: carry-out y published
+//   a = (epoch << 2 | state) << 32 | bits(c or y)      state 1: aggregate map published as its count c of finite
+//                                                      samples (gain (1 - alpha)^c) and o, 2: carry-out y published
 //   b = (epoch << 2 | 1)     << 32 | bits(o)
 struct FmScanSlot {
     unsigned long long a, b;
@@ -99,13 +101,13 @@ struct FmNarrowParams {
     float ref, alpha;
     uint32_t epoch;
     uint32_t lookback;      // predecessor tiles of finite samples after which (1 - alpha)^n < 2^-31, clamped to 1..32
+    float log2_keep;        // log2(1 - alpha) from F64, at least -1e30: the gain of c finite samples is exp2(c log2_keep)
 };
 
 template <bool DEEMPH, bool VEC>
 __global__ void __launch_bounds__(kFmTileThreads, DEEMPH ? 6 : 8) fm_narrow_fused_kernel(const FmNarrowParams p) {
-    __shared__ float warp_g[kFmTileThreads / 32], warp_o[kFmTileThreads / 32];
+    __shared__ float warp_c[kFmTileThreads / 32], warp_o[kFmTileThreads / 32];
     const uint32_t t = threadIdx.x, lane_id = t & 31, warp = t >> 5;
-    const float keep = 1.0f - p.alpha;
     for (uint64_t id = blockIdx.x; id < p.items; id += gridDim.x) {
         // id = ((frame * tiles_per_row) + tile) * lanes + lane
         const uint64_t lane = id % p.lanes;
@@ -160,47 +162,58 @@ __global__ void __launch_bounds__(kFmTileThreads, DEEMPH ? 6 : 8) fm_narrow_fuse
         float y_start = 0.0f;
         if constexpr (DEEMPH) {
             // ---- 2. this thread's map, then the tile-wide scan of map compositions ---------------------------------
-            float g = 1.0f, o = 0.0f;
+            // A map's gain is (1 - alpha)^c for the c finite samples it covers, and the scans carry c, not the gain:
+            // every gain is evaluated once from its count as exp2(c log2(1 - alpha)) with log2(1 - alpha) from F64
+            // (relative error ~1e-7 for any c). A product of F32 gains compounds one rounding per factor, and the
+            // factors of a steady stream are all the same number, so the errors add up instead of cancelling: the
+            // rounding of fl(1 - alpha) (up to 2^-25) taken 2048 times, or of a once-rounded (1 - alpha)^8 taken 256
+            // times, is 1e-5 on the gain of a tile at 20 MHz with 75 us, which put the de-emphasised output 25 ulps
+            // off, three times the reference's own F32 error. Counts are exact in F32 (< 2^24); a known carry is the
+            // constant map of count +inf (gain 0). gain(0) == 1 for every accepted alpha: count 0 is the identity map
+            // (the look-back's start, unexamined lanes, a thread's empty prefix), so log2_keep is kept finite even where
+            // alpha rounds to 1.0f (narrow rates below ~1.2 kHz), and there gain(c >= 1) == 0 as (1 - alpha)^c is.
+            const auto gain = [&p](const float c) { return exp2f(c * p.log2_keep); };
+            float o = 0.0f, c = 0.0f;
 #pragma unroll
             for (int k = 0; k < kFmPerThread; ++k) {
                 if (s0 + k < p.frame_len && isfinite(d[k])) {
                     o = __fadd_rn(o, __fmul_rn(p.alpha, __fsub_rn(d[k], o)));
-                    g *= keep;
+                    c += 1.0f;
                 }
             }
-            float sg = g, so = o;                                  // inclusive scan inside the warp
+            float sc = c, so = o;                                  // inclusive scan inside the warp
 #pragma unroll
             for (int off = 1; off < 32; off <<= 1) {
-                const float pg = __shfl_up_sync(0xffffffffu, sg, off);
+                const float pc = __shfl_up_sync(0xffffffffu, sc, off);
                 const float po = __shfl_up_sync(0xffffffffu, so, off);
                 if (lane_id >= static_cast<uint32_t>(off)) {
-                    so = fmaf(sg, po, so);                         // later map after earlier map
-                    sg *= pg;
+                    so = fmaf(gain(sc), po, so);                   // later map after earlier map
+                    sc += pc;
                 }
             }
             __syncthreads();                                       // previous tile's shared values are consumed
             if (lane_id == 31) {
-                warp_g[warp] = sg;
+                warp_c[warp] = sc;
                 warp_o[warp] = so;
             }
             __syncthreads();
             // exclusive prefix of this thread inside the tile: (warps before) then (lanes before)
-            float eg = 1.0f, eo = 0.0f, tg = 1.0f, to = 0.0f;      // (eg, eo): warps before mine; (tg, to): whole tile
+            float ec = 0.0f, eo = 0.0f, tc = 0.0f, to = 0.0f;      // (ec, eo): warps before mine; (tc, to): whole tile
 #pragma unroll
             for (int w = 0; w < kFmTileThreads / 32; ++w) {
                 if (w == static_cast<int>(warp)) {
-                    eg = tg;
+                    ec = tc;
                     eo = to;
                 }
-                to = fmaf(warp_g[w], to, warp_o[w]);
-                tg *= warp_g[w];
+                to = fmaf(gain(warp_c[w]), to, warp_o[w]);
+                tc += warp_c[w];
             }
-            float lg = __shfl_up_sync(0xffffffffu, sg, 1), lo = __shfl_up_sync(0xffffffffu, so, 1);
+            float lc = __shfl_up_sync(0xffffffffu, sc, 1), lo = __shfl_up_sync(0xffffffffu, so, 1);
             if (lane_id == 0) {
-                lg = 1.0f;
+                lc = 0.0f;
                 lo = 0.0f;
             }
-            const float xg = lg * eg, xo = fmaf(lg, eo, lo);       // map of everything before this thread in the tile
+            const float xg = gain(lc + ec), xo = fmaf(gain(lc), eo, lo);   // map of everything before this thread
 
             // ---- 3. decoupled look-back by warp 0: 32 predecessors per round, nearest first -----------------------------
             // A predecessor that already knows its carry-out y is the constant map (0, y) and ends the search. So does a
@@ -211,26 +224,26 @@ __global__ void __launch_bounds__(kFmTileThreads, DEEMPH ? 6 : 8) fm_narrow_fuse
             FmScanSlot* const mine = p.slots + id;
             if (t == 0) {
                 st_slot(&mine->b, pack_slot((p.epoch << 2) | 1u, to));
-                st_slot(&mine->a, pack_slot((p.epoch << 2) | 1u, tg));
+                st_slot(&mine->a, pack_slot((p.epoch << 2) | 1u, tc));
             }
-            __syncthreads();                                         // warp_g / warp_o of step 2 consumed by every thread
+            __syncthreads();                                         // warp_c / warp_o of step 2 consumed by every thread
             if (warp == 0) {
-                float ag = 1.0f, ao = 0.0f;                          // map of the tiles looked at so far (nearest applied last)
+                float ac = 0.0f, ao = 0.0f;                          // map of the tiles looked at so far (nearest applied last)
                 // first round: only as many predecessors as a stream of finite samples needs for the gain to vanish
                 // (p.lookback, 1 for time constants up to ~95 samples): waiting on 32 neighbours that are all in flight
                 // makes every tile as slow as the slowest of them
                 uint32_t width = p.lookback;
                 for (uint64_t back = 1;; back += width, width = 32) {
                     const uint64_t steps = back + lane_id;
-                    float mg, mo;
+                    float mc, mo;
                     bool is_carry;
                     if (lane_id >= width) {                          // not examined this round: identity
                         is_carry = false;
-                        mg = 1.0f;
+                        mc = 0.0f;
                         mo = 0.0f;
                     } else if (steps * p.lanes > id) {               // before the lane's first tile: the carried state
                         is_carry = true;
-                        mg = 0.0f;
+                        mc = __int_as_float(0x7f800000);
                         mo = p.state[lane].deemphasis;
                     } else {
                         const FmScanSlot* const slot = p.slots + (id - steps * p.lanes);
@@ -240,31 +253,31 @@ __global__ void __launch_bounds__(kFmTileThreads, DEEMPH ? 6 : 8) fm_narrow_fuse
                         }
                         is_carry = ((a >> 32) & 3u) == 2u;
                         if (is_carry) {
-                            mg = 0.0f;
+                            mc = __int_as_float(0x7f800000);
                             mo = __uint_as_float(static_cast<uint32_t>(a));
                         } else {
                             unsigned long long b = ld_slot(&slot->b);
                             while (static_cast<uint32_t>(b >> 34) != p.epoch) {
                                 b = ld_slot(&slot->b);
                             }
-                            mg = __uint_as_float(static_cast<uint32_t>(a));
+                            mc = __uint_as_float(static_cast<uint32_t>(a));
                             mo = __uint_as_float(static_cast<uint32_t>(b));
                         }
                     }
                     // warp total, nearest (lowest lane) applied last: cur = cur o (cur of lane + off)
 #pragma unroll
                     for (int off = 1; off < 32; off <<= 1) {
-                        const float fg = __shfl_down_sync(0xffffffffu, mg, off);
+                        const float fc = __shfl_down_sync(0xffffffffu, mc, off);
                         const float fo = __shfl_down_sync(0xffffffffu, mo, off);
                         if (lane_id + off < 32) {
-                            mo = fmaf(mg, fo, mo);
-                            mg *= fg;
+                            mo = fmaf(gain(mc), fo, mo);
+                            mc += fc;
                         }
                     }
-                    const float wg = __shfl_sync(0xffffffffu, mg, 0), wo = __shfl_sync(0xffffffffu, mo, 0);
-                    ao = fmaf(ag, wo, ao);
-                    ag *= wg;
-                    if (__any_sync(0xffffffffu, is_carry) || fabsf(ag) < 4.6566129e-10f) {
+                    const float wc = __shfl_sync(0xffffffffu, mc, 0), wo = __shfl_sync(0xffffffffu, mo, 0);
+                    ao = fmaf(gain(ac), wo, ao);
+                    ac += wc;
+                    if (__any_sync(0xffffffffu, is_carry) || gain(ac) < 4.6566129e-10f) {
                         break;
                     }
                 }
@@ -276,7 +289,7 @@ __global__ void __launch_bounds__(kFmTileThreads, DEEMPH ? 6 : 8) fm_narrow_fuse
             const float ao = warp_o[0];
             const float carry = ao;                                  // composed gain 0 or < 2^-31: a constant map
             if (t == 0) {
-                const float y_out = fmaf(tg, carry, to);
+                const float y_out = fmaf(gain(tc), carry, to);
                 st_slot(&mine->a, pack_slot((p.epoch << 2) | 2u, y_out));
                 // (the lane's new state is taken from its last tile's slot by fm_state_update_kernel AFTER this kernel:
                 // tiles still looking back may read state[lane].deemphasis until the very end)
@@ -998,6 +1011,15 @@ static int run_scan(const System& sys, float* thread_prefix, float* tile_agg, co
     return B200_SUCCESS;
 }
 
+// Pilot NCO phases of samples n0 .. n0 + len - 1 since reset into phase[0 .. len) (orbit-table plans only).
+static int launch_nco_phases(const b200_fm_plan* plan, float* phase, uint64_t n0, uint64_t len, cudaStream_t s) {
+    const uint64_t quads = (len + 3) / 4;
+    fm_wide_phase_table_kernel<<<static_cast<unsigned>((quads + 255) / 256), 256, 0, s>>>(
+        phase, plan->nco_checkpoints, n0, len, plan->nco_pre, plan->nco_cycle, plan->wc.pilot_phase_increment);
+    B200_LAUNCH_CHECK();
+    return B200_SUCCESS;
+}
+
 // Launch of the one-pass narrow kernel (discriminator, optional de-emphasis). `out` may be any F32 [frames, lanes, T].
 static int launch_narrow_fused(b200_fm_plan* plan, const float2* x, float* out, uint64_t frames, uint64_t frame_len,
                                bool deemph, cudaStream_t s) {
@@ -1029,6 +1051,9 @@ static int launch_narrow_fused(b200_fm_plan* plan, const float2* x, float* out, 
                                 -std::log1p(-static_cast<double>(plan->alpha));
         const double tiles_needed = per_tile > 0.0 ? std::ceil(21.5 / per_tile) : 32.0;
         q.lookback = static_cast<uint32_t>(std::min(32.0, std::max(1.0, tiles_needed)));
+        // alpha == 1.0f gives log2(0) = -inf and 0 * -inf = NaN for the identity map: clamp to a finite -1e30, for
+        // which c = 0 still gives exp2(-0) = 1 and c >= 1 gives 0
+        q.log2_keep = static_cast<float>(std::max(std::log2(1.0 - static_cast<double>(plan->alpha)), -1e30));
     }
     const bool vec = frame_len % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0 &&
                      (reinterpret_cast<uintptr_t>(out) & 15) == 0;
@@ -1224,14 +1249,13 @@ int b200_fm_exec(b200_fm_plan* plan, const b200_cf32* x, float* out, uint64_t fr
             return B200_ERROR;
         }
         if (plan->nco_cycle != 0) {
-            const uint64_t quads = (lane_len + 3) / 4;
-            fm_wide_phase_table_kernel<<<static_cast<unsigned>((quads + 255) / 256), 256, 0, s>>>(
-                phase, plan->nco_checkpoints, plan->nco_samples, lane_len, plan->nco_pre, plan->nco_cycle,
-                plan->wc.pilot_phase_increment);
+            if (launch_nco_phases(plan, phase, plan->nco_samples, lane_len, s) != B200_SUCCESS) {
+                return B200_ERROR;
+            }
         } else {
             fm_wide_phase_kernel<<<1, 32, 0, s>>>(phase, phase_state, lane_len, plan->wc.pilot_phase_increment);
+            B200_LAUNCH_CHECK();
         }
-        B200_LAUNCH_CHECK();
         plan->nco_samples += lane_len;
         const unsigned ucap = static_cast<unsigned>(cap);
         PilotSystem pilot{sum, phase, diff, at, plan->wc.pilot_alpha};
@@ -1283,6 +1307,16 @@ int b200_fm_plan_destroy(b200_fm_plan* plan) {
     cudaFree(plan->nco_checkpoints);
     delete plan;
     return B200_SUCCESS;
+}
+
+int b200_fm_nco_phases(b200_fm_plan* plan, uint64_t n0, uint64_t len, float* out, b200_stream stream) {
+    B200_REQUIRE(plan && plan->wide && plan->nco_cycle != 0, "b200_fm_nco_phases: needs a wideband plan with an NCO orbit");
+    if (len == 0) {
+        return B200_SUCCESS;
+    }
+    B200_REQUIRE(out, "b200_fm_nco_phases: null buffer");
+    DeviceGuard guard(plan->ctx);
+    return launch_nco_phases(plan, out, n0, len, as_stream(stream));
 }
 
 /* Host-only twin of the wideband pilot NCO bookkeeping (walk_nco_orbit + the fold of fm_wide_phase_table_kernel): the

@@ -403,6 +403,11 @@ int b200_fm_plan_destroy(b200_fm_plan* plan);
  * samples n0 .. n0 + len - 1 since reset, reconstructed from the orbit table the plan uses on the device instead of a
  * serial walk (the F32 state is periodic: *pre transient samples, then *cycle samples repeating). out may be NULL. */
 int b200_fm_nco_phases_host(float sample_rate, uint64_t n0, uint64_t len, float* out, uint64_t* pre, uint64_t* cycle);
+/* Test / diagnostic hook: the same phases generated on the device by the kernel b200_fm_exec uses, for a wideband
+ * plan: out is a device buffer of len F32 (a wrong fold moves a phase by a few ulps, below what the demodulated output
+ * can show, so tests compare these bit for bit with b200_fm_nco_phases_host). b200_fm_exec takes the phases of its samples from n0 = the number of samples per lane it has
+ * demodulated since the plan's creation or last reset. */
+int b200_fm_nco_phases(b200_fm_plan* plan, uint64_t n0, uint64_t len, float* out, b200_stream stream);
 
 #ifdef __cplusplus
 }

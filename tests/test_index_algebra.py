@@ -555,8 +555,9 @@ def test_fm_wide_nco_orbit_table_reproduces_the_serial_walk():
     """The wideband pilot NCO is an F32 running sum with wrap (fm/module_impl_native_cpu.cc:172-175). Its state is
     one float and the update is input independent, so the sequence is eventually periodic; the plan walks the orbit
     once and regenerates any slice in parallel (fm_wide_phase_table_kernel). Host twin of that bookkeeping
-    (b200_fm_nco_phases_host) against a plain serial F32 walk, for three sample rates, at the stream start, across
-    the transient / period boundary and many periods later."""
+    (b200_fm_nco_phases_host) against a plain serial F32 walk, for sample rates from 200 kHz to 20 MHz (1.024 MHz has a
+    transient of 5 M samples before its period), at the stream start, across the transient / period boundary and many
+    periods later."""
     import ctypes
     from cyberether_b200 import _native
     lib = _native.load()
@@ -574,7 +575,7 @@ def test_fm_wide_nco_orbit_table_reproduces_the_serial_walk():
                 ph = np.float32(np.float64(ph) - two_pi)
         return out
 
-    for rate in (250e3, 200e3, 1.2e6):
+    for rate in (250e3, 200e3, 1.2e6, 240e3, 1.024e6, 2.4e6, 20e6):
         inc = np.float32(np.float32(2.0) * np.float64(3.14159265358979323846) * np.float32(19e3) / np.float32(rate))
         pre, cycle = ctypes.c_uint64(), ctypes.c_uint64()
         head = np.empty(60000, np.float32)
