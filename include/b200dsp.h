@@ -225,7 +225,17 @@ int b200_cast_int(b200_ctx* ctx, const void* in, int in_dtype, void* out, uint64
  * 2..8: fft_generic_kernel); n = 16384 / 32768 / 65536 run TWO fused kernels over the tiled two-pass plan (window in the
  * column pass, amplitude / range in the row pass; any batch <= or > max_batch, processed in 64 MB chunks). Any other
  * length runs the module sequence multiply -> fft -> amplitude -> range through a plan-owned scratch (exec must then
- * use batch == max_batch). */
+ * use batch == max_batch).
+ * Amplitude domain of the dB output (the epilogue forms |X|^2 in F32 before an approximate square root, and adds no
+ * branch for either limit):
+ *   |X| > sqrt(F32 max) ~ 1.8e19 (a coherent CF32 tone of about 1e16 per sample): |X|^2 overflows to +inf and the bin
+ *     reads 20 ApproxLog10(2^128) + amp_coeff ~ 770.6 dB + amp_coeff, where the reference gives 20 log10|X| + amp_coeff,
+ *     300 to 400 dB lower;
+ *   2^-75 < |X| < 2^-63 ~ 1.1e-19: |X|^2 is subnormal, the square root flushes it to zero and the bin reads
+ *     20 ApproxLog10(2^-127) + amp_coeff ~ -764.6 dB + amp_coeff; below about 2^-75 |X|^2 is 0 and the bin reads -inf.
+ * The range output saturates to 1.0 above and to 0.0 below either way. Integer inputs cannot reach the upper limit.
+ * A NaN sample makes its row's spectrum NaN, and every bin of that row then reads 20 ApproxLog10((1 - 2^-24) 2^129) +
+ * amp_coeff ~ 776.7 dB + amp_coeff (range: 1.0) where the reference gives NaN. */
 int b200_chain_plan_create(b200_ctx* ctx, uint64_t n, uint64_t max_batch, const b200_cf32* window_dev,
                            b200_chain_plan** plan);
 int b200_chain_exec(b200_chain_plan* plan, const b200_cf32* x, float* out, uint64_t batch,
@@ -253,8 +263,15 @@ int b200_chain_exec_agc(b200_chain_plan* plan, const void* x, int in_dtype, floa
  * of every output column (the first loop of LineplotImplNativeCpu::computeSubmit,
  * src/domains/visualization/lineplot/module_impl_native_cpu.cc:93-98). n = 4096 with a real window and CF32 / CI8 / CU8 /
  * CI16 / CU16 input: the running sums are kept in the kernel's registers (two extra FADD per output pair); every other
- * plan runs the chain and then the row-split column-sum kernel. Reassociated F32 sum (CTA-partial order), reproducible
- * run to run. Feed colsum to b200_lineplot_update_from_colsum. */
+ * plan runs the chain and then the row-split column-sum kernel. Feed colsum to b200_lineplot_update_from_colsum.
+ * The sums are F32 in a fixed order, so they are reproducible run to run (a reassociation of the reference's
+ * sequential sum over the batch):
+ *   fused form: CTA b of G = min(batch, 2 SMs) adds out rows b, b + G, b + 2G, ... in that order, starting from +0;
+ *     then colsum[e] = partial[0][e] + partial[1][e] + ... + partial[G-1][e], in that order, starting from +0;
+ *   row-split form (dense aligned rows): splits = max(1, min(ceil(4 SMs / column_blocks), ceil(batch / 64))) with
+ *     column_blocks = ceil(n / 1024); split s adds rows s R ... min(batch, (s + 1) R) - 1 in order from +0, with
+ *     R = ceil(batch / splits); colsum[e] adds the splits in order 0 ... splits - 1 from +0.
+ * batch == 0 sets colsum to +0. */
 int b200_chain_exec_colsum(b200_chain_plan* plan, const void* x, int in_dtype, float* out, uint64_t batch, float amp_coeff,
                            int enable_range, float scale, float offset, float* colsum, b200_stream stream);
 

@@ -490,7 +490,7 @@ def _schedule_races(program):
                 tma.append((e[1], e[2], interval, pos))
             else:
                 by_element[interval, e[1], e[2]].append((tid, e[0] == "w", epoch))
-                if e[1] != "x1":
+                if e[1].startswith("stage"):
                     stage_access.append((tid, interval, pos, int(e[1][-1])))
     races = []
     for (interval, buf, elem), acc in by_element.items():
@@ -750,3 +750,173 @@ def test_fused_real_unpack_thread_assignment():
         last_pass_reads = "stage" if passes % 2 == 1 else "x1"          # pass q reads the stage buffer for even q
         zbuf = "x1" if passes % 2 == 1 else "stage"
         assert zbuf != last_pass_reads
+
+
+# ---- fft4096_kernel: shared-memory schedule across consecutive rows, and the forms the dispatch reaches ------------
+def _fft4096_kernel_code():
+    """fft4096_kernel's source from its signature on, comments removed."""
+    with open(os.path.join(CSRC, "fft4096.cuh")) as f:
+        text = f.read()
+    return re.sub(r"//[^\n]*", "", text[text.index("fft4096_kernel(const FftParams p)"):])
+
+
+def _c_eval(expr, names):
+    """Value of a C integer expression of the kernel (?:, &&, ||, comparisons, bit operators, unsigned literals)."""
+    expr = re.sub(r"\b(\d+)u\b", r"\1", expr.strip())
+    while expr.startswith("("):
+        depth = 0
+        for j, ch in enumerate(expr):
+            depth += {"(": 1, ")": -1}.get(ch, 0)
+            if depth == 0:
+                break
+        if j != len(expr) - 1:
+            break
+        expr = expr[1:-1].strip()
+    depth, question = 0, None
+    for j, ch in enumerate(expr):
+        depth += {"(": 1, ")": -1}.get(ch, 0)
+        if depth == 0 and ch == "?" and question is None:
+            question, nested = j, 0
+        elif depth == 0 and question is not None and ch == "?":
+            nested += 1
+        elif depth == 0 and question is not None and ch == ":":
+            if nested == 0:
+                branch = expr[question + 1:j] if _c_eval(expr[:question], names) else expr[j + 1:]
+                return _c_eval(branch, names)
+            nested -= 1
+    python = expr.replace("&&", " and ").replace("||", " or ")
+    return eval(re.sub(r"!(?!=)", " not ", python), {"__builtins__": {}}, dict(names))
+
+
+def _fft4096_schedule_expressions(code):
+    """The index expressions of the kernel's cross-row reuse, read from its source."""
+    find = lambda pattern: re.search(pattern, code).group(1)
+    return {"buf": find(r"buf = smem_raw \+ \(([^;]*)\) \* kFft4096StageBytes;"),
+            "land": find(r"land = smem_raw \+ kLandBase \+ ([^;]*) \* kLandPitch;"),
+            "refill_if": find(r"if \(t == 0 && ([^{]*)\) \{\s*const uint32_t slot"),
+            "slot": find(r"const uint32_t slot = ([^;]*);"),
+            "agc_write": find(r"agc_partial\[([^\]]*)\]\[t >> 5\] = power;"),
+            "agc_read": find(r"mean_power \+= agc_partial\[([^\]]*)\]\[w\];")}
+
+
+_FFT4096_SYNCTHREADS = 3        # after the mbarrier init, (A) and (C)
+
+
+def _fft4096_kernel_schedule(exprs, integer, stages, agc, rows):
+    """Program order of every thread of one fft4096_kernel CTA over its first `rows` rows, in the event format of
+    _radix_kernel_schedule. CF32: the row lands in stage{s}, which is also its exchange buffer. Integer input: the row lands
+    in stage{s} of the landing ring and the exchanges use xchg{0|1}. agc{0|1}[warp] are the AGC partials. Elements are
+    float2 slots (landing slots of integer rows: samples). Split barrier (B) is a barrier at its arrive point."""
+    my_rows = rows + stages
+    program = []
+    for t in range(256):
+        lo4, hi4 = t & 15, t >> 4
+        ev, issued = [("sync",)], 0
+
+        def issue(slot):
+            nonlocal issued
+            if issued < my_rows:
+                if t == 0:
+                    ev.append(("tma", slot, issued))
+                issued += 1
+
+        for s in range(stages):
+            issue(s)
+        stage = refill_stage = 0
+        for i in range(rows):
+            names = {"kInt": integer, "i": i, "stage": stage, "refill_stage": refill_stage, "issued": issued,
+                     "my_rows": my_rows}
+            buf = f"{'xchg' if integer else 'stage'}{_c_eval(exprs['buf'], names)}"
+            land = f"stage{_c_eval(exprs['land'], names)}"
+            ev.append(("wait", i))
+            ev += [("r", land if integer else buf, t + 256 * a) for a in range(16)]       # pass 1 loads
+            if agc and t % 32 == 0:
+                ev.append(("w", f"agc{_c_eval(exprs['agc_write'], names)}", t >> 5))
+            ev += [("w", buf, t + 256 * k) for k in range(16)]                            # pass 1 stores
+            ev.append(("sync",))                                                           # (A)
+            if _c_eval(exprs["refill_if"], names):
+                issue(_c_eval(exprs["slot"], names))
+            ev += [("r", buf, 256 * hi4 + lo4 + 16 * b) for b in range(16)]               # exchange-1 reads
+            ev.append(("sync",))                                                           # (B)
+            ev += [("w", buf, 18 * hi4 + lo4 + 288 * k) for k in range(16)]               # exchange-2 stores
+            ev.append(("sync",))                                                           # (C)
+            ev += [("r", buf, 18 * lo4 + 288 * hi4 + c) for c in range(16)]               # pass 3 (LDS.128 pairs)
+            if agc:
+                ev += [("r", f"agc{_c_eval(exprs['agc_read'], names)}", w) for w in range(8)]
+            refill_stage = stage
+            stage = (stage + 1) % stages
+        program.append(ev)
+    return program
+
+
+def test_fft4096_kernel_schedule_is_race_free_across_consecutive_rows():
+    """fft4096_kernel is persistent and reuses shared memory from row to row: the CF32 ring (refilled after barrier (A)
+    with the row kStages ahead, into the previous row's stage), the integer landing ring (refilled with the current row's
+    slot), the two exchange buffers of integer input (alternating by row parity), and the AGC partials (by row parity).
+    The replay covers stages + 3 consecutive rows of one CTA for CF32 with 3 stages (2 CTAs/SM, with AGC), CF32 with 2
+    stages (3 CTAs/SM) and integer input with 3 x 8 KiB and 2 x 16 KiB landing rings (with AGC), and checks with
+    _schedule_races that every pair of accesses that could race is ordered.
+
+    The schedule is a hand restatement of fft4096.cuh; the index expressions of the reuse (exchange buffer, landing slot,
+    refill condition and slot, AGC partial rows) are read from the kernel source, and the source's __syncthreads count
+    must match the restatement. Split barrier (B) is modelled as a barrier at its arrive point, which is exact because
+    the code between mbar_arrive(reads_done) and mbar_wait(reads_done, ...) only calls register-only helpers."""
+    code = _fft4096_kernel_code()
+    exprs = _fft4096_schedule_expressions(code)
+    between = code[code.index("mbar_arrive(reads_done);") + len("mbar_arrive(reads_done);"):code.index("mbar_wait(reads_done")]
+    assert set(re.findall(r"(\w+)\s*\(", between)) <= {"dft16_rest", "apply_twiddles"}, between
+    assert not re.search(r"\b(buf|land|smem_raw|agc_partial|full|reads_done)\b|\[", between), between
+    assert code.count("__syncthreads()") == _FFT4096_SYNCTHREADS
+    failures = []
+    for name, integer, stages, agc in (("CF32, 3 stages", False, 3, True), ("CF32, 2 stages", False, 2, False),
+                                       ("8-bit, 3 x 8 KiB", True, 3, True), ("16-bit, 2 x 16 KiB", True, 2, True)):
+        races = _schedule_races(_fft4096_kernel_schedule(exprs, integer, stages, agc, stages + 3))
+        if races:
+            failures.append(f"{name}: {len(races)} races, e.g. {races[0]}")
+    assert not failures, "\n".join(failures)
+
+
+def test_fft4096_c_expressions_evaluate_as_in_c():
+    names = {"kInt": False, "i": 3, "stage": 2, "refill_stage": 1, "issued": 4, "my_rows": 9}
+    assert _c_eval("kInt ? (i & 1u) : stage", names) == 2
+    assert _c_eval("kInt ? stage : refill_stage", names) == 1
+    assert _c_eval("(kInt || i >= 1) && issued < my_rows", names)
+    assert _c_eval("i & 1", dict(names, i=4)) == 0
+    assert _c_eval("kInt ? (i & 1u) : stage", dict(names, kInt=True)) == 1
+
+
+def _fft_cu_dispatch_forms():
+    """(entry point, MODE, WIN, ITYPE) of every fft4096_kernel form fft.cu's default dispatch reaches at n = 4096."""
+    with open(os.path.join(CSRC, "fft.cu")) as f:
+        src = f.read()
+    # launch_4096_int always runs the real-window kernel, launch_fft runs fft4096_kernel for every window at n = 4096
+    assert "auto kernel = fft4096_kernel<MODE, WIN_REAL, 2, ITYPE, AGC, COLSUM>;" in src
+    launch_fft = src[src.index("static int launch_fft("):]
+    assert re.search(r"if \(p\.n == kFft4096N && MODE != MODE_C2C[^{]*\{\s*return launch_4096<MODE, WIN>",
+                     launch_fft[:launch_fft.index("try_launch_radix")])
+    entries = {"B200_CHAIN_DISPATCH": "chain_exec", "B200_INT_DISPATCH": "chain_exec_typed",
+               "B200_AGC_DISPATCH": "chain_exec_agc", "B200_COLSUM_DISPATCH": "chain_exec_colsum"}
+    flags = {"chain_exec_typed": "", "chain_exec_agc": ", true", "chain_exec_colsum": ", false, true"}
+    forms = set()
+    for macro, entry in entries.items():
+        region = src[src.index(f"#define {macro}(MODE)"):src.index(f"#undef {macro}")]
+        body, uses = region[:region.index("if (enable_range)")], region[region.index("if (enable_range)"):]
+        modes = re.findall(rf"{macro}\((MODE_\w+)\)", uses)
+        if entry == "chain_exec":
+            kinds = [(w, "IN_CF32") for w in re.findall(r"launch_fft<MODE, (WIN_\w+)>", body)]
+        else:
+            launches = re.findall(r"launch_4096_int<MODE, (IN_\w+)((?:, (?:true|false))*)>", body)
+            assert all(f == flags[entry] for _, f in launches), (macro, launches)
+            kinds = [("WIN_REAL", t) for t, _ in launches]
+        forms |= {(entry, m, w, t) for m in modes for w, t in kinds}
+    return forms
+
+
+def test_chain_forms_table_is_the_fft4096_dispatch_and_every_form_has_a_gpu_case():
+    import chain_forms
+    import test_gpu_chain_forms as gpu
+    assert len(chain_forms.FORMS) == len(set(chain_forms.FORMS)) == 34
+    assert _fft_cu_dispatch_forms() == set(chain_forms.FORMS)
+    marks = [m for m in gpu.test_chain_form_steady_state.pytestmark if m.name == "parametrize"]
+    assert len(marks) == 1 and marks[0].args[1] is gpu.CASES
+    assert [c.values[0] for c in gpu.CASES] == chain_forms.FORMS
